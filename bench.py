@@ -22,7 +22,7 @@ JSON line (one, from rank 0):
              the unmodified PyTorch application experiences it (host<->device
              copies, map/unmap, scan, protocol and scheduling all inside)
   iter_per_s oversubscribed-client iterations per second over the timed window
-  roofline   the dominant sm_100a kernel of the timed region against the measured
+  roofline   the dominant sm_90a kernel of the timed region against the measured
              peak that bounds it: at N=1 the scan/hash kernel (HBM-bound; the bytes
              themselves cross PCIe on the copy engines -- `roofline_link` has both
              directions against the link peak measured in this run); at N>1 the
@@ -60,6 +60,9 @@ from pathlib import Path
 
 ROOT = Path(__file__).resolve().parent
 sys.path.insert(0, str(ROOT))
+# nothing is written into the tree at run time (it may be read-only): no bytecode caches, here or in the clients
+sys.dont_write_bytecode = True
+os.environ["PYTHONDONTWRITEBYTECODE"] = "1"
 
 from nvshare_b200 import harness  # noqa: E402
 
@@ -87,8 +90,15 @@ def parse_args():
                          "arm needs fits the box's limit, else the largest fraction that does")
     ap.add_argument("--no-extras", action="store_true", help="skip the same_scale / configs sub-runs")
     ap.add_argument("--keep", default="", help="directory to keep logs in")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps every client writes a fixed, seeded sample of the output it computed "
+                         "in its last step and of its inputs to DIR/client<i>_{z,x,y,index}.npy (add and matmul); the "
+                         "inputs follow from the arguments and the HBM fraction (--hbm-fraction pins it across boxes)")
     ap.add_argument("--probe", action="store_true", help=argparse.SUPPRESS)
-    return ap.parse_args()
+    args = ap.parse_args()
+    if args.dump_outputs and args.kind not in ("add", "matmul"):
+        ap.error("--dump-outputs is implemented for --kind add and matmul")
+    return args
 
 
 def dist_env():
@@ -145,15 +155,33 @@ def measure_peer_peak(torch, nbytes=4 * GiB):
     return out
 
 
-def hbm_peak():
-    try:
-        return float(json.load(open(ROOT / "MEASURED_PEAKS.json"))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (burst)"
-    except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+def measure_hbm_peak(torch, nbytes=4 * GiB):
+    """HBM read + write traffic of b.copy_(a) device-to-device, CUDA events, best of 3: the roofline
+    denominator for the HBM-bound kernels, measured on this GPU in this run."""
+    a = torch.empty(nbytes, dtype=torch.uint8, device="cuda")
+    b = torch.empty(nbytes, dtype=torch.uint8, device="cuda")
+    b.copy_(a)
+    best = 0.0
+    for _ in range(3):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        b.copy_(a)
+        e1.record()
+        e1.synchronize()
+        best = max(best, 2 * nbytes / 1e6 / e0.elapsed_time(e1))
+    del a, b
+    torch.cuda.empty_cache()
+    return best
 
 
-def measure_kernels(torch, nbytes=4 * GiB):
-    """The sm_100a kernels alone, through the C-ABI: the TMA slab copy device-to-device on all SMs (shows the
+def hbm_peak(probe):
+    if probe.get("hbm_copy_GBps"):
+        return probe["hbm_copy_GBps"], "b.copy_(a) device-to-device (read + write traffic) measured in this run"
+    return 3350.0, "H100 SXM data sheet (HBM3), not measured in this run"
+
+
+def measure_kernels(torch, peak, source, nbytes=4 * GiB):
+    """The sm_90a kernels alone, through the C-ABI: the TMA slab copy device-to-device on all SMs (shows the
     link, not the kernel, bounds the NVLink/PCIe path) and the scan/hash kernel over the same bytes."""
     from nvshare_b200 import engine as E
     src = torch.empty(nbytes, dtype=torch.uint8, device="cuda")
@@ -171,7 +199,6 @@ def measure_kernels(torch, nbytes=4 * GiB):
         same = all(a == b for a, b in zip(scans[0][0], scans[1][0]))
     del src, dst
     torch.cuda.empty_cache()
-    peak, source = hbm_peak()
     traffic_gbps = 2 * nbytes / 1e6 / ms            # every payload byte is read once and written once
     return {"copy_d2d": {"bound": "hbm", "kernel": "nvs_slab_copy_tma (device-to-device, %d CTAs)" % n_sms,
                          "achieved": traffic_gbps, "peak": peak, "unit": "GB/s", "frac": traffic_gbps / peak,
@@ -187,10 +214,10 @@ def probe_main():
     torch.zeros(1, device="cuda")
     free_b, total_b = torch.cuda.mem_get_info()
     out = {"hbm_free": free_b, "hbm_total": total_b, "n_gpus_visible": torch.cuda.device_count(),
-           "link": measure_link_peak(torch), "peer": measure_peer_peak(torch)}
+           "link": measure_link_peak(torch), "peer": measure_peer_peak(torch), "hbm_copy_GBps": measure_hbm_peak(torch)}
     if os.environ.get("NVS_BENCH_PROBE_KERNELS", "1") == "1":
         try:
-            out["kernels"] = measure_kernels(torch)
+            out["kernels"] = measure_kernels(torch, *hbm_peak(out))
         except Exception as ex:      # no engine library: report it, the bench itself will fail loudly later
             out["kernels_error"] = repr(ex)
     print("PROBE " + json.dumps(out), flush=True)
@@ -206,25 +233,6 @@ def run_probes(kernels=True):
         if line.startswith("PROBE "):
             return json.loads(line[6:])
     raise SystemExit("probe subprocess failed:\n" + r.stdout[-2000:] + r.stderr[-3000:])
-
-
-def ncu_traffic_ratios():
-    """DRAM bytes (read + write) per algorithmic byte of our kernels, from the committed `ncu --set full`
-    captures (profiles/r02_ncu_traffic.json, written by tools/ncu_summarise.py; r01 capture as a fallback)."""
-    try:
-        return json.load(open(ROOT / "profiles" / "r02_ncu_traffic.json"))
-    except Exception:
-        pass
-    import csv
-    try:
-        rows = list(csv.reader(open(ROOT / "profiles" / "r01_ncu_full_tma_selected.csv")))
-        hdr, first = rows[0], rows[2]
-        rd = float(first[hdr.index("dram__bytes_read.sum")])
-        wr = float(first[hdr.index("dram__bytes_write.sum")])
-        return {"nvs_slab_copy_tma": {"dram_per_algorithmic_byte": (rd + wr) * 1e9 / float(1 << 30),
-                                      "source": "profiles/r01_ncu_full_tma_selected.csv (1 GiB HBM -> host launch)"}}
-    except Exception:
-        return {}
 
 
 def cpu_baseline(sample_gib=4):
@@ -259,7 +267,7 @@ def cpu_baseline(sample_gib=4):
 
 def host_memory_budget():
     """Bytes of host RAM this job may still take: the cgroup limit (pinned and UVM
-    host pages are charged to it: profiles/r01_probe_h_pinned_accounting.txt) or MemAvailable."""
+    host pages are charged to it) or MemAvailable."""
     avail = None
     try:
         for line in open("/proc/meminfo"):
@@ -279,7 +287,7 @@ def host_memory_budget():
 
 
 def host_memory_needed(impl, clients, footprint, hbm_avail, world=1):
-    """What each arm keeps in host RAM (measured, r01 call 3): the reference's UVM ends up
+    """What each arm keeps in host RAM: the reference's UVM ends up
     holding every client's pages on the host.  Ours: the shared pool is a budget fixed at creation
     (one HBM's worth, cut to what the cgroup / tmpfs allow: engine.c shp_open) -- what is swapped out
     is the floor it needs; kept copies use whatever else the budget has.  Peer tier: next to nothing."""
@@ -351,20 +359,22 @@ def statistics_mean(xs):
 
 
 def run_experiment(impl, kind, pattern, clients, oversub, tq, warmup, steps, total_b, hbm_fraction, world, out_dir,
-                   peer_capacity_frac=0.92, time_limit_s=None):
+                   peer_capacity_frac=0.92, time_limit_s=None, dump=None):
     """One co-located run: calibration (solo, un-hooked), the clients under the chosen library + scheduler,
     analysis.  Returns a dict; never raises for a failed run (reports it)."""
     out_dir = Path(out_dir)
     out_dir.mkdir(parents=True, exist_ok=True)
     hbm_avail = int(total_b * hbm_fraction)
     spec, footprint = make_spec(kind, pattern, oversub * hbm_avail / clients)
+    if dump:
+        spec["dump"] = str(dump)
     # what MUST come in (and go out) per hand-off: the arriving client's working set minus the share of the
     # HBM the holder does not need -- at best all of that share belongs to the client whose turn is next
     algo_bytes_dir = max(min(footprint, 2 * footprint - hbm_avail), 0.0)
     res = {"kind": kind, "impl": impl, "clients": clients, "tq_s": tq, "steps": steps, "warmup": warmup,
            "hbm_fraction_used": hbm_fraction, "footprint_bytes_per_client": footprint,
            "oversubscription": clients * footprint / hbm_avail, "algorithmic_bytes_per_handoff_per_direction": algo_bytes_dir,
-           "spec": {k: v for k, v in spec.items() if k != "golden"}}
+           "spec": {k: v for k, v in spec.items() if k not in ("golden", "dump")}}
 
     ballast = None
     if hbm_fraction < 0.999:
@@ -495,28 +505,22 @@ def run_experiment(impl, kind, pattern, clients, oversub, tq, warmup, steps, tot
 def roofline_objects(exp, probe, world):
     """The `roofline` family of keys from one experiment of our arm."""
     d = exp.get("device") or {}
-    traffic = ncu_traffic_ratios()
     link = probe["link"]
     out = {}
     scan_launches = max(d.get("evicts", 0), 1)
-    hbm_pk, hbm_src = hbm_peak()
+    hbm_pk, hbm_src = hbm_peak(probe)
     scan = {"bound": "hbm", "kernel": "nvs_slab_scan", "achieved": d.get("scan_GBps"), "peak": hbm_pk, "unit": "GB/s",
             "frac": d["scan_GBps"] / hbm_pk if d.get("scan_GBps") else None, "peak_source": hbm_src,
             "algorithmic_bytes_total": d.get("bytes_scanned"),
             "note": "bytes the scan/hash launches of the timed evictions read / their CUDA-event time; alone on an idle GPU: "
                     "see roofline_kernels.scan_hash.  The peak is the measured COPY figure (read + write traffic of b.copy_(a)); "
                     "a read-only pass has no write turn-arounds and can exceed it (frac > 1)"}
-    t = traffic.get("nvs_slab_scan")
-    per_launch = d["bytes_scanned"] / d["scan_launches"] if d.get("scan_launches") else None
-    scan["algorithmic_bytes_per_launch"] = per_launch
+    scan["algorithmic_bytes_per_launch"] = d["bytes_scanned"] / d["scan_launches"] if d.get("scan_launches") else None
     scan["launches"] = d.get("scan_launches")
-    scan["traffic"] = per_launch * t["dram_per_algorithmic_byte"] if t and per_launch else None
-    scan["traffic_source"] = (f"DRAM read + write bytes per launch = algorithmic bytes per launch x {t['dram_per_algorithmic_byte']:.4f} "
-                              f"({t['source']})") if t else None
     if world == 1:
         out["roofline"] = scan
         out["roofline_link"] = {
-            "bound": "pcie", "engine": "copy engines (cuMemcpyAsync), both directions: 256-byte TLPs, probes D/G",
+            "bound": "pcie", "engine": "copy engines (cuMemcpyAsync), both directions",
             "evict": {"achieved": d.get("evict_GBps"), "peak": link["d2h"],
                       "frac": d["evict_GBps"] / link["d2h"] if d.get("evict_GBps") else None},
             "fetch": {"achieved": d.get("fetch_GBps"), "peak": link["h2d"],
@@ -528,22 +532,16 @@ def roofline_objects(exp, probe, world):
         pk_out, pk_in = peer.get("out"), peer.get("in")
         per_dir = [g for g in (d.get("evict_GBps"), d.get("fetch_GBps")) if g]
         achieved = sum(per_dir) / len(per_dir) if per_dir else None
-        pk = (pk_out + pk_in) / 2 if pk_out and pk_in else 770.0
-        t = traffic.get("nvs_slab_copy_tma")
+        pk = (pk_out + pk_in) / 2 if pk_out and pk_in else None
         out["roofline"] = {"bound": "nvlink", "kernel": "nvs_slab_copy_tma", "achieved": achieved, "peak": pk, "unit": "GB/s",
-                           "frac": achieved / pk if achieved else None,
+                           "frac": achieved / pk if achieved and pk else None,
                            "evict": {"achieved": d.get("evict_GBps"), "peak": pk_out,
                                      "frac": d["evict_GBps"] / pk_out if d.get("evict_GBps") and pk_out else None},
                            "fetch": {"achieved": d.get("fetch_GBps"), "peak": pk_in,
                                      "frac": d["fetch_GBps"] / pk_in if d.get("fetch_GBps") and pk_in else None},
-                           "peak_source": "cuMemcpyPeer GPU0<->GPU1 measured in this run" if pk_out else
-                                          "770 GB/s (B200_PROFILING.md fallback)",
+                           "peak_source": "cuMemcpyPeer GPU0<->GPU1 measured in this run" if pk_out else "not measured",
                            "algorithmic_bytes_per_launch": ((d["peer_bytes"]["out"] + d["peer_bytes"]["in"]) / d["copy_kernel_launches"]
-                                                            if d.get("copy_kernel_launches") else None),
-                           "traffic": ((d["peer_bytes"]["out"] + d["peer_bytes"]["in"]) / d["copy_kernel_launches"] * t["dram_per_algorithmic_byte"]
-                                       if t and d.get("copy_kernel_launches") else None),
-                           "traffic_source": (f"local DRAM bytes per launch = algorithmic bytes per launch x {t['dram_per_algorithmic_byte']:.4f} "
-                                              f"({t['source']})") if t else None}
+                                                            if d.get("copy_kernel_launches") else None)}
         out["roofline_scan"] = scan
     out["roofline_kernels"] = probe.get("kernels")
     return out
@@ -610,7 +608,8 @@ def run_rank0(args, world):
     out_dir = Path(args.keep) if args.keep else Path(tempfile.mkdtemp(prefix="nvs_bench_"))
     t0 = time.time()
     exp = run_experiment(args.impl, args.kind, args.pattern, args.clients, args.oversub, args.tq, args.warmup, args.steps,
-                         total_b, frac, world if args.impl == "ours" else 1, out_dir / "main")
+                         total_b, frac, world if args.impl == "ours" else 1, out_dir / "main",
+                         dump=Path(args.dump_outputs).resolve() if getattr(args, "dump_outputs", "") else None)
     _, _, _, ref_script = KIND_DEFAULTS[args.kind]
     sp = exp["spec"]
     what = (f"fp32 [n,n] n={sp['n']} ({args.pattern})" if "n" in sp else
@@ -629,7 +628,7 @@ def run_rank0(args, world):
             "hbm_bytes": total_b, "hbm_fraction_used": frac, "scale_note": scale_note,
             "backing_tier": "peer-HBM over NVLink (GPUs 1..%d) + pinned host" % (world - 1) if world > 1 and args.impl == "ours"
                             else "pinned host DRAM over PCIe Gen5 x16",
-            "l2_policy": "inputs (>= tens of GB per hand-off) exceed the 126 MB L2",
+            "l2_policy": "inputs (>= tens of GB per hand-off) exceed the 50 MB L2",
             "algorithmic_bytes_per_handoff_per_direction": exp["algorithmic_bytes_per_handoff_per_direction"],
             "host_cores": ncpu,
         },
@@ -709,9 +708,9 @@ def brief(exp):
     return out
 
 
-# The driver gives every `bench.py --gpus N` run 870 s (SCALE_r01.json per_n_timeout_s); the sub-runs only get
-# what the headline has left of a budget well inside that, and say so when they had to be skipped or cut.
-TOTAL_BUDGET_S = 780.0
+# A `bench.py --gpus N` run has to finish inside 10 minutes; the sub-runs only get what the headline has left
+# of a budget well inside that, and say so when they had to be skipped or cut.
+TOTAL_BUDGET_S = 480.0
 
 
 def extras(args, line, probe, world, total_b, frac, out_dir, t_bench_start):

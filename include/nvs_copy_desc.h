@@ -1,6 +1,6 @@
 /*
  * nvs_copy_desc.h -- the one data structure shared by the host engine (C) and
- * the sm_100a slab-copy kernels (CUDA).
+ * the sm_90a slab-copy kernels (CUDA).
  *
  * A descriptor is one contiguous byte move of at most one slab (2 MiB) between
  * two device-addressable ranges: local HBM (a cuMemMap'd chunk of a hooked
@@ -23,7 +23,7 @@
 #include <stdint.h>
 
 #define NVS_SLAB_SHIFT 21u
-#define NVS_SLAB_BYTES (1ull << NVS_SLAB_SHIFT) /* 2 MiB: B200 VMM granule and TLB page */
+#define NVS_SLAB_BYTES (1ull << NVS_SLAB_SHIFT) /* 2 MiB: the VMM granule and TLB page */
 
 typedef struct nvs_copy_desc {
 	uint64_t src;   /* device-addressable source address      */

@@ -1,5 +1,5 @@
 /*
- * nvshare_engine.h -- C-ABI of the B200 swap engine: the explicit
+ * nvshare_engine.h -- C-ABI of the H100 swap engine: the explicit
  * prefetch/evict data path that replaces the reference's one-line data path
  *
  *     real_cuMemAllocManaged(dptr, bytesize, CU_MEM_ATTACH_GLOBAL)
@@ -43,14 +43,14 @@
  *                    "this process, device 0" to "every process, per GPU" (SURVEY 8e)
  *   nvs_touch        no counterpart (recency hint from the hooked cuMemcpy / cuMemset calls)
  *   nvs_copy_slabs / nvs_scan_slabs / nvs_pattern_fill / nvs_pattern_verify
- *                    no counterpart: raw access to the sm_100a kernels for the
+ *                    no counterpart: raw access to the sm_90a kernels for the
  *                    parity tests and the roofline measurement
  *
  * Return values: 0 on success, otherwise a CUresult value from the driver
  * (2 = CUDA_ERROR_OUT_OF_MEMORY, 3 = CUDA_ERROR_NOT_INITIALIZED, ...) or one
  * of the negative NVS_E_* codes below.  No device copy ever falls back to the
  * CPU: if the driver or the kernel image cannot be loaded, creation fails, and
- * bytes that are in HBM only move by the sm_100a kernels / copy engines.
+ * bytes that are in HBM only move by the sm_90a kernels / copy engines.
  * (nvs_host_io is not such a fallback: both ends of its copies are host RAM.)
  */
 #ifndef NVSHARE_ENGINE_H
@@ -66,7 +66,7 @@ extern "C" {
 #define NVS_E_NOT_OURS   (-2) /* pointer was not allocated by this engine          */
 #define NVS_E_BAD_ARG    (-3)
 #define NVS_E_NO_DRIVER  (-4) /* libcuda.so.1 or a required entry point is missing */
-#define NVS_E_NO_KERNEL  (-5) /* embedded sm_100a image failed to load             */
+#define NVS_E_NO_KERNEL  (-5) /* embedded sm_90a image failed to load             */
 #define NVS_E_TIMEOUT    (-6) /* HBM did not become available in time              */
 #define NVS_E_HOST_OOM   (-7) /* backing tier exhausted                            */
 #define NVS_E_SHUTDOWN   (-8) /* the CUDA context is being destroyed (process exit) */
@@ -119,7 +119,7 @@ typedef struct nvs_engine_config {
 	uint32_t elide_constant;
 	/* a fetch that needs HBM somebody else is still releasing waits while the free HBM keeps
 	 * growing and starts mapping when it has stood still for a few ms, or when this many bytes
-	 * (64 GiB) are free: release and create calls of two processes must not interleave (probe K) */
+	 * (64 GiB) are free: release and create calls of two processes must not interleave */
 	uint64_t burst_bytes;
 	/* 1 = keep the backing copy of a chunk after it has been fetched (as long as the pool has
 	 * room: retained units are the first to be reclaimed), record a 128-bit hash per slab when a
@@ -150,7 +150,7 @@ typedef struct nvs_xfer_report {
 	uint64_t clean_bytes;  /* evict: slabs whose retained backing copy was still valid
 	                          (hash unchanged): swapped out without being copied      */
 	uint64_t ce_calls;     /* cuMemcpyAsync calls (copy engines); `launches` counts
-	                          sm_100a kernel launches only                            */
+	                          sm_90a kernel launches only                            */
 	uint64_t scanned_bytes; /* bytes the scan/hash kernel read from HBM                */
 	double   scan_ms;      /* CUDA-event time of the scan/hash launches               */
 	uint64_t scan_launches; /* how many of `launches` were scan/hash launches          */

@@ -3,9 +3,9 @@
   build_product()  nvshare_b200/csrc/Makefile -> nvshare_b200/_build/
                    {libnvshare.so, libnvs_engine.so, nvshare-scheduler, nvsharectl,
                     slab_copy.cubin}; the only CUDA TU is compiled with
-                   -gencode arch=compute_100a,code=sm_100a -lineinfo
+                   -gencode arch=compute_90a,code=sm_90a -lineinfo
   build_oracle()   oracle/Makefile -> oracle/_ref/ (test infrastructure: the
-                   unmodified reference when /root/reference is present, the fake
+                   unmodified reference where its sources can be read, the fake
                    driver, the C restatement, the test applications, and the
                    reference's hook + client bound to our C-ABI: libnvshare_bound.so)
 """
@@ -60,4 +60,4 @@ def build_oracle() -> Path:
 
 
 def reference_available() -> bool:
-    return all((ORACLE_OUT / n).exists() for n in ("libnvshare.so", "nvshare-scheduler", "nvsharectl"))
+    return all((ORACLE_OUT / n).exists() for n in ("libnvshare.so", "nvshare-scheduler", "nvsharectl", "libsockdir.so"))

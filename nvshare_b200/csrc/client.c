@@ -136,7 +136,7 @@ void nvs_client_pressure(uint64_t mib)
 
 static uint64_t evict_margin_mib(void)
 {
-	/* 1/512 of the HBM (357 MiB on a B200): covers the 64 MiB of slack the fetching side wants to
+	/* 1/512 of the HBM (160 MiB on an 80 GB H100): covers the 64 MiB of slack the fetching side wants to
 	 * see free beyond what it maps (engine.c wait_for_hbm_burst) and the context growth of a client
 	 * that starts using a library between two hand-offs.  Every MiB of it crosses the link twice per
 	 * hand-off for nothing, hence no more than that (round 1 used 1/128: 1.5 GiB). */
@@ -350,9 +350,9 @@ static void *message_thread(void *arg)
 				uint64_t mib = strtoull(in.data + 1, NULL, 10);
 				sync_app_context();
 				/* At least FAVOUR_MIN_MIB at a time: a framework that is building its state allocates
-				 * thousands of blocks, each of which stalls ~0.3 s before it presses (r2 call 5: a
-				 * ResNet-50 client took 260 s to set up beside an idle one that gave way 1 GiB at a
-				 * time).  We do not hold the lock: whatever goes now comes back with our next fetch. */
+				 * thousands of blocks, each of which stalls before it presses (a ResNet-50 client
+				 * took minutes to set up beside an idle one that gave way 1 GiB at a time).  We do not
+				 * hold the lock: whatever goes now comes back with our next fetch. */
 				if (mib && mib < FAVOUR_MIN_MIB)
 					mib = FAVOUR_MIN_MIB;
 				do_evict_as_a_favour(mib ? mib + evict_margin_mib() : EVICT_ALL);

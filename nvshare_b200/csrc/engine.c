@@ -1,17 +1,16 @@
 /*
- * engine.c -- the B200 swap engine (host side, plain C on the CUDA driver API).
+ * engine.c -- the H100 swap engine (host side, plain C on the CUDA driver API).
  *
  * The reference has no such component: its whole data path is one call,
  * real_cuMemAllocManaged() (reference src/hook.c:673), after which NVIDIA's
  * UVM driver migrates pages on GPU faults.  This file is that data path made
- * explicit and B200-shaped:
+ * explicit and H100-shaped:
  *
  *   allocation  cuMemAddressReserve for the application's pointer (stable for
  *               the allocation's life) + cuMemCreate/cuMemMap/cuMemSetAccess
  *               per CHUNK (default 256 MiB = 128 slabs).  VMM calls cost per call,
- *               not per byte (profiles/r01_probe_b200.txt section B: mapping
- *               8 GiB = 221 ms in 2 MiB units, 6.7 ms in 64 MiB, 2.0 ms in
- *               256 MiB).  Copy and accounting granularity stays one SLAB (2 MiB).
+ *               not per byte (tools/probe.cu section B measures it per
+ *               mapping-chunk size).  Copy and accounting granularity stays one SLAB (2 MiB).
  *   backing     tier 1: HBM of peer GPUs (cuMemCreate on the peer, mapped into
  *               this context; striped per chunk; arenas returned as soon as they
  *               are empty; no NCCL).  tier 0: pinned host DRAM -- by default ONE
@@ -24,8 +23,8 @@
  *               nvs_slab_copy_tma on a side stream, batch b+1 copying while
  *               batch b is unmapped and its HBM released.
  *   fetch       the mirror image with the copy engines (the evicting process is
- *               running its kernel at the same time; probe G): wait until a BURST
- *               of HBM is free (probe K), map it back to back, copy, splat the
+ *               running its kernel at the same time): wait until a BURST
+ *               of HBM is free, map it back to back, copy, splat the
  *               same-filled slabs.
  *
  * Chunk states:  UNBACKED (virtual only; contents undefined like fresh
@@ -249,9 +248,8 @@ struct arena {
  * Shared pinned-host pool: ONE backing store for every client of a scheduler
  * (a file in /dev/shm mapped by all of them), so that host RAM tracks what is
  * actually swapped out (~0.5 C for two clients at 1.5x) instead of the sum of
- * per-process pools (~1.0-1.5 C).  On the r01 box pinned memory is charged to a
- * 200 GiB cgroup (probe H), which the per-process pools of the BASELINE
- * configuration would exceed.  Layout of the file:
+ * per-process pools (~1.0-1.5 C).  Where pinned memory is charged to a memory
+ * cgroup, the per-process pools of the BASELINE configuration can exceed it.  Layout of the file:
  *   [0, SHP_HDR_BYTES)   struct shp_hdr: robust process-shared mutex, slab
  *                        bitmap, owner pid per slab
  *   [SHP_HDR_BYTES, ..)  data: capacity_slabs x 2 MiB, handed out in contiguous
@@ -278,7 +276,7 @@ struct shp_hdr {
 	 * the one that is fetching: how much HBM the eviction announced by `releaser_pid` has given
 	 * back so far.  The fetching side waits on these words instead of polling cuMemGetInfo every
 	 * millisecond -- driver calls of two processes at the moment one of them runs hundreds of
-	 * cuMemUnmap / cuMemRelease back to back are exactly what made the release slow (probe K). */
+	 * cuMemUnmap / cuMemRelease back to back are exactly what makes the release slow. */
 	volatile int32_t releaser_pid;       /* 0: nobody is releasing                           */
 	volatile uint32_t release_seq;       /* bumped at every announcement                     */
 	volatile uint64_t released_bytes;    /* since the announcement                           */
@@ -310,7 +308,7 @@ struct pool {
 
 struct scan_result;
 struct slot {
-	nvs_copy_desc *descs; /* pinned, device-mapped: what the sm_100a copy kernel consumes */
+	nvs_copy_desc *descs; /* pinned, device-mapped: what the sm_90a copy kernel consumes */
 	uint64_t descs_dev;
 	uint32_t n_descs, cap_descs;
 	nvs_copy_desc *ce;    /* plain host memory: runs handed to the copy engines            */
@@ -458,7 +456,7 @@ static int is_shutdown_error(CUresult r)
 
 const char *nvs_engine_version(void)
 {
-	return "nvshare_b200 engine r2 (sm_100a: slab copy tma|ldg, scan+hash, splat; copy engines for the PCIe tier)";
+	return "nvshare_b200 engine r2 (sm_90a: slab copy tma|ldg, scan+hash, splat; copy engines for the PCIe tier)";
 }
 
 const char *nvs_strerror(int rc)
@@ -468,7 +466,7 @@ const char *nvs_strerror(int rc)
 	case NVS_E_NOT_OURS: return "pointer not owned by the engine";
 	case NVS_E_BAD_ARG: return "bad argument";
 	case NVS_E_NO_DRIVER: return "CUDA driver (libcuda.so.1) or a required entry point is missing";
-	case NVS_E_NO_KERNEL: return "embedded sm_100a kernel image failed to load";
+	case NVS_E_NO_KERNEL: return "embedded sm_90a kernel image failed to load";
 	case NVS_E_TIMEOUT: return "timed out waiting for HBM to be released";
 	case NVS_E_HOST_OOM: return "backing tier exhausted";
 	case NVS_E_SHUTDOWN: return "the CUDA context is being torn down (process exit)";
@@ -516,29 +514,25 @@ int nvs_engine_default_config(nvs_engine_config *cfg)
 	cfg->batch_bytes = env_u64("NVSHARE_BATCH_MIB", 1024) << 20;
 	cfg->burst_bytes = env_u64("NVSHARE_BURST_MIB", 65536) << 20;
 	cfg->host_arena_bytes = env_u64("NVSHARE_HOST_ARENA_MIB", 1024) << 20;
-	/* Pinned-host tier (PCIe Gen5 x16), B200 probes D and G: the copy engines move 55.4 (out) /
-	 * 55.2 (in) GB/s alone and 50.2 + 48.7 with both directions busy in two processes; the
-	 * sm_100a kernel 52.7 / 51.5 alone (SM-issued transfers travel as 128-byte TLPs) and, being
-	 * compute work, is time-sliced against the other process's kernel (22 + 22).  So both
-	 * directions of this tier run on the copy engines; the SMs scan, hash and splat.
-	 * Peer tier (NVLink 5): the kernel (3.3 TB/s device-to-device against 0.5 TB/s of
-	 * per-chunk cuMemcpyAsync) for both directions.
+	/* Pinned-host tier (PCIe Gen5 x16): the copy engines carry 256-byte TLPs, SM-issued transfers
+	 * 128-byte ones, and the copy kernel, being compute work, is time-sliced against the other
+	 * process's kernel.  So both directions of this tier run on the copy engines; the SMs scan,
+	 * hash and splat.  Peer tier (NVLink): the kernel, which keeps many more bytes in flight than
+	 * per-chunk cuMemcpyAsync calls, for both directions.
 	 * NVSHARE_COPY_VARIANT sets all four; the specific variables override it. */
 	const char *all = getenv("NVSHARE_COPY_VARIANT");
 	cfg->evict_variant = parse_variant(getenv("NVSHARE_EVICT_VARIANT"), parse_variant(all, NVS_COPY_CE));
 	cfg->fetch_variant = parse_variant(getenv("NVSHARE_FETCH_VARIANT"), parse_variant(all, NVS_COPY_CE));
 	cfg->peer_evict_variant = parse_variant(getenv("NVSHARE_PEER_EVICT_VARIANT"), parse_variant(all, NVS_COPY_TMA));
 	/* ... except that a FETCH usually runs while the previous holder's eviction kernel is still going
-	 * in another process, and the GPU time-slices kernels of different processes (probe G: 22 + 22
-	 * GB/s kernel + kernel against 49 + 44 kernel + copy engine): eviction kernel + fetch on the copy
+	 * in another process, and the GPU time-slices kernels of different processes: eviction kernel + fetch on the copy
 	 * engines overlap, two kernels take turns.  NVSHARE_PEER_FETCH_VARIANT=tma for a fetch that has
 	 * the GPU to itself. */
 	cfg->peer_fetch_variant = parse_variant(getenv("NVSHARE_PEER_FETCH_VARIANT"), parse_variant(all, NVS_COPY_CE));
 	cfg->retain = (uint32_t)env_u64("NVSHARE_RETAIN", 1);
 	cfg->preclean = (uint32_t)env_u64("NVSHARE_PRECLEAN", 1);
-	/* B200 probe: 2 CTAs already saturate PCIe Gen5 x16 in one direction
-	 * (52.7 GB/s); 8 leaves head-room when SMs are shared; the peer tier
-	 * (NVLink 5) wants ~74. */
+	/* 0 = derived per launch (grid_for()): 8 CTAs for the PCIe tier, with head-room for SMs that
+	 * are shared with a client's kernels, and half the SMs for the peer tier. */
 	cfg->copy_grid = (uint32_t)env_u64("NVSHARE_COPY_GRID", 0);
 	cfg->tma_warps = (uint32_t)env_u64("NVSHARE_TMA_WARPS", 1);
 	cfg->tma_stages = (uint32_t)env_u64("NVSHARE_TMA_STAGES", 6);
@@ -622,10 +616,8 @@ static int parse_cpulist(const char *s, cpu_set_t *set)
  */
 static void numa_init(nvs_engine *e, CUdevice dev, nvs_resolve_fn resolve)
 {
-	/* Opt-in (NVSHARE_NUMA=1).  Measured on the r01 boxes (two sockets, profiles/r01_call18_*,
-	 * r01_call19_*): eviction 43.7 / fetch 51.9 GB/s with every page on the GPU's node versus
-	 * 44.3 / 52.0 GB/s with two thirds of them on the other one -- the socket interconnect is
-	 * not the bottleneck there, so the default stays what all other measurements were taken with. */
+	/* Opt-in (NVSHARE_NUMA=1): on a two-socket box the socket interconnect is not the bottleneck of
+	 * a PCIe transfer, so the default leaves the pages where the kernel puts them. */
 	const char *sw = getenv("NVSHARE_NUMA");
 	if (!(sw && *sw && atoi(sw) != 0))
 		return;
@@ -1493,7 +1485,7 @@ static int shp_open(nvs_engine *e, const char *path, uint64_t capacity_bytes)
 		/* Whoever creates the pool fixes its capacity, and with kept copies the pool WILL fill up
 		 * to it.  A tmpfs smaller than the pool (docker's default /dev/shm is 64 MiB) would turn
 		 * page faults into SIGBUS, a memory cgroup smaller than it (pinned and tmpfs pages are
-		 * charged to it: profiles/r01_probe_h_pinned_accounting.txt) into an OOM kill: shrink the
+		 * charged to it) into an OOM kill: shrink the
 		 * budget to what the box can really give, and only fall back to private pools when that
 		 * is less than a quarter of what was asked for. */
 		char dir[256];
@@ -1789,7 +1781,7 @@ static int chunk_map_ex(nvs_engine *e, struct chunk *c, double *wait_ms, int whi
 		}
 		/* Wait until the driver reports room for this chunk before trying again: a
 		 * failing cuMemCreate is expensive and serialises with the cuMemRelease
-		 * calls of the process that is evicting (measured: B200 r01 call 2). */
+		 * calls of the process that is evicting. */
 		pthread_mutex_unlock(&e->mu); /* api_mu still serialises the entry points; let stats / pinning run */
 		for (int spin = 0; spin < 20; ++spin) {
 			size_t free_b = 0, total_b = 0;
@@ -1906,11 +1898,10 @@ static void mask_fill(uint64_t *m, uint32_t n)
 		mask_set(m, i);
 }
 
-/* Which engine moves a chunk between HBM and its backing tier?  Measured on B200 (probes D, G):
- * over PCIe a copy-engine transfer carries 256-byte TLPs, an SM-issued one 128-byte TLPs --
- * 55.4 vs 52.7 GB/s alone, 50+49 vs 49+44 with both directions busy -- so the pinned-host tier
- * moves on the copy engines and the SMs do what those cannot (scan, hash, splat).  Over NVLink
- * the kernel wins (3.3 TB/s device-to-device against 0.5 TB/s of per-chunk cuMemcpyAsync). */
+/* Which engine moves a chunk between HBM and its backing tier?  Over PCIe a copy-engine transfer
+ * carries 256-byte TLPs, an SM-issued one 128-byte TLPs, so the pinned-host tier moves on the copy
+ * engines and the SMs do what those cannot (scan, hash, splat).  Over NVLink the kernel, which keeps
+ * many more bytes in flight than per-chunk cuMemcpyAsync calls, moves both directions. */
 /* one launch consumes the whole kernel list of a slot: the peer tier's kernel if it has one */
 static uint32_t kernel_variant(const nvs_engine *e, int to_backing)
 {
@@ -1965,7 +1956,7 @@ static int slot_push_chunk(nvs_engine *e, struct slot *s, struct chunk *c, int t
 	return 0;
 }
 
-/* Enqueue everything a slot has gathered on e->stream: one sm_100a kernel launch for the
+/* Enqueue everything a slot has gathered on e->stream: one sm_90a kernel launch for the
  * kernel list, one cuMemcpyAsync per run of the copy-engine list. */
 static int slot_launch(nvs_engine *e, struct slot *s, uint32_t kernel_variant, nvs_xfer_report *rep)
 {
@@ -2469,10 +2460,9 @@ out:
 /*
  * Burst gating.  While another process is still handing its HBM back, do NOT map
  * each chunk the moment it fits: with HBM full, one process releasing and another
- * creating chunk by chunk slow every VMM call from ~0.2 ms to ~5 ms (B200, probe K:
- * 41 GB/s of "hand-over bandwidth", less than the PCIe copy it is supposed to feed);
- * one process at a time runs at ~0.2 ms per call (511 GB/s with 8 GiB bursts, 1.2 TB/s
- * for a releaser left alone).  Round 1 therefore mapped in fixed 8 GiB bursts.
+ * creating chunk by chunk slow every VMM call down by an order of magnitude, below the
+ * PCIe copy it is supposed to feed; one process at a time runs at full speed.  Round 1
+ * therefore mapped in fixed 8 GiB bursts.
  *
  * Round 2: since unchanged slabs are no longer copied, most of an eviction is a bare
  * release that takes ~0.1 s for 70 GB -- if nobody interferes.  So the gate now follows
@@ -3539,7 +3529,7 @@ int nvs_engine_create(const nvs_engine_config *cfg_in, nvs_engine **out)
 	    e->d.ModuleGetFunction(&e->fn_verify, e->module, "nvs_slab_verify") != CUDA_SUCCESS ||
 	    e->d.ModuleGetFunction(&e->fn_scan, e->module, "nvs_slab_scan") != CUDA_SUCCESS ||
 	    e->d.ModuleGetFunction(&e->fn_splat, e->module, "nvs_slab_splat") != CUDA_SUCCESS) {
-		nvs_warn("engine: the embedded sm_100a image could not be loaded on this device");
+		nvs_warn("engine: the embedded sm_90a image could not be loaded on this device");
 		rc = NVS_E_NO_KERNEL;
 		goto out;
 	}

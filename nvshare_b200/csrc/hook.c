@@ -601,7 +601,7 @@ static nvs_engine *engine_get(void)
 			nvs_engine *made = NULL; /* published below: lock-free readers (lent_now, the copy bypass) load `engine` atomically */
 			int rc = nvs_engine_create(&cfg, &made);
 			if (rc == NVS_E_NO_KERNEL || rc == NVS_E_NO_DRIVER) {
-				/* not a B200 (only the sm_100a image is embedded), or a driver without the VMM entry
+				/* not an H100 (only the sm_90a image is embedded), or a driver without the VMM entry
 				 * points: the drop-in still has to work, so this process runs on the reference's
 				 * managed-memory mechanism (cuMemAllocManaged + UVM faults) like NVSHARE_ENGINE=uvm */
 				nvs_warn("swap engine unavailable on this GPU/driver (%s): falling back to the reference's "

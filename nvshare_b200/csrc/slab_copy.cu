@@ -1,5 +1,5 @@
 /*
- * slab_copy.cu -- the hot kernel of the B200 swap engine (sm_100a only).
+ * slab_copy.cu -- the hot kernel of the H100 swap engine (sm_90a only).
  *
  * What it replaces: in the reference, the bytes of an oversubscribed
  * allocation move between HBM and host DRAM inside NVIDIA's UVM driver, one
@@ -25,7 +25,7 @@
  *                       can read pinned host and peer memory as well).
  *   nvs_slab_fill       writes that pattern.
  *
- * Bound: link bandwidth (PCIe Gen5 x16 or NVLink 5), not HBM and not tensor
+ * Bound: link bandwidth (PCIe Gen5 x16 or NVLink 4), not HBM and not tensor
  * cores -- see DESIGN.md.  Work is distributed dynamically (one atomicAdd per
  * descriptor) so CTAs that share an SM with a client's kernels simply take
  * fewer slabs.
@@ -242,7 +242,7 @@ nvs_slab_copy_ldg(const nvs_copy_desc *__restrict__ descs, uint32_t n_descs, uin
 
 /*
  * Two ways of not moving a slab at all, both decided by ONE pass of the SMs over it
- * at HBM speed (~120x the PCIe link, ~9x NVLink) -- the copy engines cannot do either:
+ * at HBM speed (tens of times the PCIe link, several times NVLink) -- the copy engines cannot do either:
  *
  *  - same-filled: all 64-bit words equal (zero-initialised buffers, ones(), padding,
  *    memset workspaces -- the reference's own test tensors are torch.ones): 8 bytes
@@ -274,8 +274,8 @@ nvs_slab_copy_ldg(const nvs_copy_desc *__restrict__ descs, uint32_t n_descs, uin
  * 64-bit sums over the lanes.  Consequences: ANY change confined to one lane's stream
  * (in particular any single-word change) is detected with certainty; changes spread
  * over several lanes escape with probability ~2^-128.  12 integer instructions per
- * 16 bytes: the pass stays HBM-bound (148 SMs x 128 lanes x 1.9 GHz / 12 x 16 B = 48 TB/s
- * of hashing capacity against 6.5-7.7 TB/s of HBM).
+ * 16 bytes: the pass stays HBM-bound (132 SMs x 128 lanes x 1.98 GHz / 12 x 16 B = 45 TB/s
+ * of hashing capacity against the 3.35 TB/s of HBM3 the H100 SXM data sheet gives).
  */
 struct nvs_scan_result {
 	unsigned long long value;

@@ -1,7 +1,7 @@
 """ctypes mirror of include/nvshare_engine.h (libnvs_engine.so).
 
 Host-side plumbing only: every call lands in the C engine, which launches the
-sm_100a slab-copy kernels.  There is no Python or CPU fallback here -- if the
+sm_90a slab-copy kernels.  There is no Python or CPU fallback here -- if the
 shared library is missing or fails to initialise, these functions raise.
 
 Reference interface mirrored: the engine stands where the reference has the
@@ -248,7 +248,7 @@ class Engine:
 
 
 def scan_slabs(engine: Engine, descs, want_hash=True, with_ms=False):
-    """nvs_scan_slabs: run the sm_100a scan/hash kernel over (src, _, nbytes) ranges."""
+    """nvs_scan_slabs: run the sm_90a scan/hash kernel over (src, _, nbytes) ranges."""
     descs = list(descs)
     arr = (CopyDesc * max(len(descs), 1))()
     for i, (s, _d, b) in enumerate(descs):

@@ -22,10 +22,12 @@ from __future__ import annotations
 
 import json
 import os
+import shutil
 import signal
 import statistics
 import subprocess
 import sys
+import tempfile
 import time
 from pathlib import Path
 
@@ -37,6 +39,14 @@ REF = ROOT / "oracle" / "_ref"
 def impl_paths(impl: str):
     base = BUILD if impl == "ours" else REF
     return {"lib": base / "libnvshare.so", "sched": base / "nvshare-scheduler", "ctl": base / "nvsharectl"}
+
+
+def preload_for(impl, lib):
+    """LD_PRELOAD for a process of `impl`: the reference's binaries only know /var/run/nvshare, which an ordinary
+    user cannot create; oracle/_ref/libsockdir.so, in front of them, takes NVSHARE_SOCK_DIR instead."""
+    first = [] if impl == "ours" else [str(REF / "libsockdir.so")]
+    rest = [os.environ["LD_PRELOAD"]] if os.environ.get("LD_PRELOAD") else []
+    return ":".join(first + [str(lib)] + rest) if lib else ":".join(first + rest)
 
 
 # ----------------------------------------------------------------- analysis --
@@ -146,9 +156,9 @@ def engine_records(paths, t_start, t_end):
 # ------------------------------------------------------------------ running --
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md).  Once a second:
+    """nvidia-smi clocks / throttle reasons during the timed region.  Once a second:
     every sample is a round of NVML queries that take driver locks the hand-off's cuMemUnmap /
-    cuMemCreate calls also need (r2 call 5: the same 373 unmaps took 150 ms or 1.4 s)."""
+    cuMemCreate calls also need."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -198,8 +208,9 @@ def start_scheduler(impl, sock_dir, log_path, tq, debug=True, cpus=None):
         env["NVSHARE_DEBUG"] = "1"
     else:
         env.pop("NVSHARE_DEBUG", None)
-    if impl == "ours":
-        env["NVSHARE_SOCK_DIR"] = str(sock_dir)
+    env["NVSHARE_SOCK_DIR"] = str(sock_dir)
+    if impl != "ours":
+        env["LD_PRELOAD"] = preload_for(impl, None)
     sock = Path(sock_dir) / "scheduler.sock"
     if sock.exists():
         sock.unlink()
@@ -219,6 +230,13 @@ def start_scheduler(impl, sock_dir, log_path, tq, debug=True, cpus=None):
     return p
 
 
+def sock_dir_for(out_dir):
+    """Where the daemon listens: out_dir/sock unless the socket's path would not fit a Unix socket address
+    (107 bytes), then a fresh directory under /tmp."""
+    d = Path(out_dir) / "sock"
+    return d if len(str(d / "scheduler.sock")) <= 107 else Path(tempfile.mkdtemp(prefix="nvs-sock-", dir="/tmp"))
+
+
 def scheduler_pingpong(impl, out_dir, clients=2, cycles=20000, trials=5):
     """BASELINE config #1 (CPU only): the daemon of `impl` and `clients` scripted clients that do nothing but
     REQ_LOCK -> LOCK_OK -> LOCK_RELEASED (tools/pingpong.c, the same binary against both daemons).  No GPU, no
@@ -236,7 +254,7 @@ def scheduler_pingpong(impl, out_dir, clients=2, cycles=20000, trials=5):
         raise RuntimeError(f"{tool} is missing: run __graft_entry__.build()")
     out_dir = Path(out_dir)
     out_dir.mkdir(parents=True, exist_ok=True)
-    sock_dir = out_dir / "sock" if impl == "ours" else Path("/var/run/nvshare")
+    sock_dir = sock_dir_for(out_dir)
     sock_dir.mkdir(parents=True, exist_ok=True)
     env = dict(os.environ)
     env.pop("LD_PRELOAD", None)
@@ -260,6 +278,8 @@ def scheduler_pingpong(impl, out_dir, clients=2, cycles=20000, trials=5):
                 runs.append(json.loads(r.stdout.strip().splitlines()[-1]))
         finally:
             stop_process(sched)
+            if sock_dir.parent != out_dir:
+                shutil.rmtree(sock_dir, ignore_errors=True)
         runs.sort(key=lambda x: x["handoffs_per_s"])
         med = runs[len(runs) // 2]
         out[name] = {"handoffs_per_s": med["handoffs_per_s"], "req_to_lock_ok_us": med["req_to_lock_ok_us"],
@@ -294,6 +314,8 @@ def client_cmd(spec, log, tag, barrier="", stop_file="", seconds=0.0, extra=()):
     if spec["kind"] in ("add", "matmul"):
         cmd = [sys.executable, "-m", "nvshare_b200.workloads", "--kind", spec["kind"], "--n", str(spec["n"]),
                "--iters", str(spec.get("iters", 100000000)), "--pattern", spec["pattern"]]
+        if spec.get("dump"):
+            cmd += ["--dump-outputs", str(spec["dump"])]
     else:
         cmd = [sys.executable, "-m", "nvshare_b200.workloads_models", "--kind", spec["kind"],
                "--steps", str(spec.get("steps", 6)), "--batch", str(spec.get("batch", 16)), "--tf32", str(spec.get("tf32", 0))]
@@ -321,7 +343,7 @@ def calibrate(spec, out_dir, env=None, timeout=1800):
     env = dict(env or os.environ, PYTHONPATH=str(ROOT) + (":" + os.environ["PYTHONPATH"] if os.environ.get("PYTHONPATH") else ""))
     env.pop("LD_PRELOAD", None)
     if spec["kind"] in ("add", "matmul"):
-        cal = dict(spec, pattern="ones", iters=spec.get("calibration_iters", 6 if spec["kind"] == "matmul" else 40))
+        cal = dict(spec, pattern="ones", iters=spec.get("calibration_iters", 6 if spec["kind"] == "matmul" else 40), dump=None)
         cmd = client_cmd(cal, log, "calibration", extra=["--no-verify"])
         golden = None
     else:
@@ -348,7 +370,7 @@ def run_clients(impl, out_dir, n_clients, spec, seconds, tq, extra_env=None, sta
     out_dir = Path(out_dir)
     out_dir.mkdir(parents=True, exist_ok=True)
     paths = impl_paths(impl)
-    sock_dir = out_dir / "sock" if impl == "ours" else Path("/var/run/nvshare")
+    sock_dir = sock_dir_for(out_dir)
     sock_dir.mkdir(parents=True, exist_ok=True)
     sched = start_scheduler(impl, sock_dir, out_dir / "scheduler.log", tq)
     barrier = out_dir / "go"
@@ -361,13 +383,13 @@ def run_clients(impl, out_dir, n_clients, spec, seconds, tq, extra_env=None, sta
         for i in range(n_clients):
             # keep whatever is already preloaded (e.g. a profiler's injection library) behind ours, and
             # whatever is on PYTHONPATH (the driver's sitecustomize hook records which .so files we load)
-            preload = str(paths["lib"]) + (":" + os.environ["LD_PRELOAD"] if os.environ.get("LD_PRELOAD") else "")
+            preload = preload_for(impl, paths["lib"])
             pypath = str(ROOT) + (":" + os.environ["PYTHONPATH"] if os.environ.get("PYTHONPATH") else "")
             env = dict(os.environ, LD_PRELOAD=preload, PYTHONPATH=pypath)
             if gpu is not None:
                 env["CUDA_VISIBLE_DEVICES"] = str(gpu)
+            env["NVSHARE_SOCK_DIR"] = str(sock_dir)
             if impl == "ours":
-                env["NVSHARE_SOCK_DIR"] = str(sock_dir)
                 env["NVSHARE_STATS_FILE"] = str(out_dir / f"engine{i}.jsonl")
             env.update({k: str(v) for k, v in (extra_env or {}).items()})
             cmd = client_cmd(spec, out_dir / f"client{i}.jsonl", f"client{i}", barrier, stop_file, seconds)
@@ -403,6 +425,8 @@ def run_clients(impl, out_dir, n_clients, spec, seconds, tq, extra_env=None, sta
             if p.poll() is None:
                 p.kill()
         stop_process(sched)
+        if sock_dir.parent != out_dir:
+            shutil.rmtree(sock_dir, ignore_errors=True)
     res = []
     for i, p in enumerate(procs):
         iters, meta = load_iters(out_dir / f"client{i}.jsonl") if (out_dir / f"client{i}.jsonl").exists() else ([], {})

@@ -57,6 +57,24 @@ def _fill_pos(torch, t, salt: int, block_rows: int, bits: int = 22):
         t[r0:r0 + r].copy_(b)
 
 
+DUMP_SAMPLES = 1 << 20
+
+
+def dump_sample(torch, out_dir, tag, tensors):
+    """The same DUMP_SAMPLES elements (seeded positions, the same for every tensor of one shape) of each
+    tensor as float32, and the positions as float64: two builds run with the same arguments can be
+    compared element for element without writing n^2 elements."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    numel = next(iter(tensors.values())).numel()
+    g = torch.Generator().manual_seed(20240917)
+    idx = torch.randint(0, numel, (min(DUMP_SAMPLES, numel),), generator=g).sort().values
+    idx_dev = idx.to(next(iter(tensors.values())).device)
+    for name, t in tensors.items():
+        np.save(os.path.join(out_dir, f"{tag}_{name}.npy"), t.reshape(-1)[idx_dev].float().cpu().numpy())
+    np.save(os.path.join(out_dir, f"{tag}_index.npy"), idx.to(torch.float64).numpy())
+
+
 def run(argv=None) -> int:
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--kind", choices=["add", "matmul"], default="add")
@@ -71,6 +89,8 @@ def run(argv=None) -> int:
     ap.add_argument("--start-barrier", default="", help="path: wait until this file exists before iterating")
     ap.add_argument("--stop-file", default="", help="path: finish the loop (then verify) once this file exists")
     ap.add_argument("--no-verify", action="store_true", help="skip the result check (timing calibration runs)")
+    ap.add_argument("--dump-outputs", default="", help="directory: after the loop, write a fixed sample of the output "
+                    "and the inputs as <tag>_{z,x,y,index}.npy")
     args = ap.parse_args(argv)
 
     import torch
@@ -137,6 +157,8 @@ def run(argv=None) -> int:
         if args.stop_file and (it & 15) == 0 and os.path.exists(args.stop_file):
             break
     t_end = time.time()
+    if args.dump_outputs and z is not None:
+        dump_sample(torch, args.dump_outputs, args.tag, {"z": z, "x": x, "y": y})
 
     # -- verification (the reference prints PASS unconditionally; we check)
     bad = 0

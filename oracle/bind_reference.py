@@ -18,6 +18,7 @@ announcement, the cap that follows what the GPU has lent) -> oracle/_ref/libnvsh
 """
 from __future__ import annotations
 
+import os
 import shutil
 import subprocess
 import sys
@@ -25,7 +26,7 @@ import tempfile
 from pathlib import Path
 
 ROOT = Path(__file__).resolve().parent.parent
-REF = Path("/root/reference")
+REF = Path(os.environ.get("REF", "/root/reference"))      # where oracle/Makefile looks too
 OUT = ROOT / "oracle" / "_ref" / "libnvshare_bound.so"
 BUILD = ROOT / "nvshare_b200" / "_build"
 
@@ -137,7 +138,7 @@ def main():
     REF = Path(sys.argv[1]) if len(sys.argv) > 1 else REF
     OUT = Path(sys.argv[2]) if len(sys.argv) > 2 else (OUT.with_name("libnvshare_bound_opt.so") if optional else OUT)
     src = REF / "src"
-    if not (src / "hook.c").exists():
+    if not os.access(src / "hook.c", os.R_OK):
         print(f"reference sources not present ({src}): nothing to bind")
         return 0
     if not (BUILD / "libnvs_engine.so").exists():

@@ -175,7 +175,7 @@ CUresult cuInit(unsigned flags)
 CUresult cuDriverGetVersion(int *v) { *v = 12090; return OK; }
 CUresult cuDeviceGetCount(int *n) { *n = getenv("FAKE_CUDA_DEVICES") ? atoi(getenv("FAKE_CUDA_DEVICES")) : 1; return OK; }
 CUresult cuDeviceGet(CUdevice *d, int ord) { *d = ord; return OK; }
-CUresult cuDeviceGetName(char *name, int len, CUdevice d) { (void)d; snprintf(name, len, "FAKE B200"); return OK; }
+CUresult cuDeviceGetName(char *name, int len, CUdevice d) { (void)d; snprintf(name, len, "FAKE H100"); return OK; }
 CUresult cuDeviceTotalMem_v2(size_t *b, CUdevice d) { (void)d; setup_once(); *b = g_total; return OK; }
 /* the UUID belongs to the physical GPU: two processes that number the GPUs differently agree on it */
 CUresult cuDeviceGetUuid_v2(unsigned char uuid[16], CUdevice d)
@@ -184,7 +184,7 @@ CUresult cuDeviceGetUuid_v2(unsigned char uuid[16], CUdevice d)
 	if (getenv("FAKE_CUDA_NO_UUID"))
 		return E_NOT_FOUND;
 	memset(uuid, 0, 16);
-	memcpy(uuid, "GPU-FAKE-B200-", 14);
+	memcpy(uuid, "GPU-FAKE-H100-", 14);
 	uuid[15] = (unsigned char)phys_of(d);
 	return OK;
 }
@@ -192,8 +192,8 @@ CUresult cuDeviceGetAttribute(int *v, int attr, CUdevice d)
 {
 	(void)d;
 	switch (attr) {
-	case 16: *v = 148; break;  /* SM count */
-	case 75: *v = 10; break;   /* cc major */
+	case 16: *v = 132; break;  /* SM count */
+	case 75: *v = 9; break;    /* cc major */
 	case 76: *v = 0; break;    /* cc minor */
 	case 102: *v = 1; break;   /* VMM supported */
 	default: *v = 1; break;
@@ -684,7 +684,7 @@ static unsigned long g_launches;
 
 CUresult cuModuleLoadData(CUmodule *m, const void *image)
 {
-	if (getenv("FAKE_CUDA_NO_BINARY")) { /* "this GPU is not sm_100a": CUDA_ERROR_NO_BINARY_FOR_GPU */
+	if (getenv("FAKE_CUDA_NO_BINARY")) { /* "this GPU is not sm_90a": CUDA_ERROR_NO_BINARY_FOR_GPU */
 		trace("cuModuleLoadData -> 209");
 		return 209;
 	}

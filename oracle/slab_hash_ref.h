@@ -1,6 +1,6 @@
 /*
  * slab_hash_ref.h -- TEST INFRASTRUCTURE ONLY.  Plain-C restatement of the 128-bit
- * content hash the sm_100a scan kernel computes per slab (nvshare_b200/csrc/
+ * content hash the sm_90a scan kernel computes per slab (nvshare_b200/csrc/
  * slab_copy.cu, nvs_slab_scan with want_hash).  Included by the oracle
  * (oracle_slab_hash: the checker of the kernel on the GPU) and by the fake driver
  * (so that the engine's clean-slab logic runs on CPU).  No reference counterpart:

@@ -18,6 +18,8 @@ ROOT = Path(__file__).resolve().parent.parent
 BUILD = Path(os.environ.get("NVS_TEST_BUILD", ROOT / "nvshare_b200" / "_build"))
 ORACLE = ROOT / "oracle" / "_ref"
 FAKE_DIR = ORACLE / "fakecuda"
+# preloaded into every reference binary: the directory NVSHARE_SOCK_DIR names instead of its fixed /var/run/nvshare
+REF_SHIM = ORACLE / "libsockdir.so"
 
 MSG_SIZE = 537
 MSG_FMT = "<B254s254sQ20s"
@@ -107,10 +109,9 @@ class Daemon:
         self.sock_dir = Path(sock_dir)
         exe = (BUILD if impl == "ours" else ORACLE) / "nvshare-scheduler"
         env = dict(os.environ)
-        if impl == "ours":
-            env["NVSHARE_SOCK_DIR"] = str(self.sock_dir)
-        else:
-            assert str(self.sock_dir).rstrip("/") == "/var/run/nvshare", "the reference has a fixed socket dir"
+        env["NVSHARE_SOCK_DIR"] = str(self.sock_dir)
+        if impl != "ours":
+            env["LD_PRELOAD"] = str(REF_SHIM)
         if debug:
             env["NVSHARE_DEBUG"] = "1"
         else:
@@ -136,9 +137,9 @@ class Daemon:
     def ctl(self, *args, impl=None, check=True):
         impl = impl or self.impl
         exe = (BUILD if impl == "ours" else ORACLE) / "nvsharectl"
-        env = dict(os.environ)
-        if impl == "ours":
-            env["NVSHARE_SOCK_DIR"] = str(self.sock_dir)
+        env = dict(os.environ, NVSHARE_SOCK_DIR=str(self.sock_dir))
+        if impl != "ours":
+            env["LD_PRELOAD"] = str(REF_SHIM)
         r = subprocess.run([str(exe), *args], env=env, capture_output=True, text=True)
         if check:
             assert r.returncode == 0, r.stderr
@@ -177,6 +178,13 @@ def fake_env(total_mib=4096, ledger=None, trace=None, devices=1, extra=None):
 
 
 def preload(lib_impl):
-    lib = str((BUILD if lib_impl == "ours" else ORACLE) / "libnvshare.so")
+    if lib_impl != "ours":
+        return with_ref_shim(ORACLE / "libnvshare.so")
+    lib = str(BUILD / "libnvshare.so")
     first = os.environ.get("NVS_TEST_PRELOAD_FIRST")
-    return f"{first}:{lib}" if first and lib_impl == "ours" else lib
+    return f"{first}:{lib}" if first else lib
+
+
+def with_ref_shim(lib):
+    """LD_PRELOAD for a library that contains the reference's client code: it connects where NVSHARE_SOCK_DIR says."""
+    return f"{REF_SHIM}:{lib}"

@@ -47,11 +47,11 @@ def test_libnvshare_exports_the_reference_boundary(artefacts):
     assert not (internals & {s.split("@")[0] for s in syms})
 
 
-@pytest.mark.reference
 def test_exports_are_a_superset_of_the_reference_binary(artefacts):
-    # driver entry points (cu + capital) and dlsym; the reference's other visible symbols
-    # (cuda_ctx, dlsym_225, ...) are accidental (no `local:` in its version script)
-    ref = {s.split("@")[0] for s in dynsyms(ORACLE / "libnvshare.so") if re.match(r"cu[A-Z]|dlsym@", s)}
+    # driver entry points (cu + capital) and dlsym, as `nm -D` lists them for the reference's libnvshare.so
+    # (tests/golden/make_golden.py); its other visible symbols (cuda_ctx, dlsym_225, ...) are accidental
+    # (no `local:` in its version script)
+    ref = set(json.loads((ROOT / "tests" / "golden" / "reference_exports.json").read_text()))
     ours = {s.split("@")[0] for s in dynsyms(BUILD / "libnvshare.so")}
     assert ref <= ours, ref - ours
 
@@ -65,12 +65,12 @@ def test_libnvshare_needs_only_libc(artefacts):
     assert "soname: [libnvshare.so]" in out                  # src/Makefile:19
 
 
-def test_kernel_image_is_sm100a_with_bulk_copies(artefacts):
+def test_kernel_image_is_sm90a_with_bulk_copies(artefacts):
     import shutil
     if not shutil.which("cuobjdump"):
         pytest.skip("cuobjdump not installed")
     sass = subprocess.run(["cuobjdump", "-sass", str(BUILD / "slab_copy.cubin")], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass or "SM100" in sass.upper()
+    assert "sm_90a" in sass or "SM90" in sass.upper()
     tma = sass.split("Function : nvs_slab_copy_tma")[1].split("Function :")[0]
     assert "UBLKCP.S.G" in tma and "UBLKCP.G.S" in tma        # cp.async.bulk both ways (TMA, non-tensor)
     assert "SYNCS.ARRIVE.TRANS64" in tma                      # mbarrier expect_tx

@@ -13,7 +13,7 @@ import sys
 
 import pytest
 
-from nvs_testlib import ORACLE, ROOT, Daemon, fake_env
+from nvs_testlib import ORACLE, ROOT, Daemon, fake_env, with_ref_shim
 
 pytestmark = pytest.mark.reference
 BOUND = ORACLE / "libnvshare_bound.so"
@@ -47,7 +47,7 @@ def test_two_oversubscribed_clients_under_the_reference_daemon(bound, default_so
             env = fake_env(total_mib=200, ledger=tmp_path / "hbm", trace=tmp_path / f"trace{i}.txt",
                            extra={"NVSHARE_HOST_ARENA_MIB": 64, "NVSHARE_CHUNK_MIB": 8, "NVSHARE_BATCH_MIB": 32, "NVSHARE_DEBUG": 1,
                                   "NVSHARE_STATS_FILE": tmp_path / f"stats{i}.jsonl"})
-            env["LD_PRELOAD"] = str(bound)
+            env["LD_PRELOAD"] = with_ref_shim(bound)
             procs.append(subprocess.Popen([str(ORACLE / "driver_app"), "40", "4.0", str(i), "3"], env=env,
                                           stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True))
         outs = [p.communicate(timeout=120) for p in procs]
@@ -90,7 +90,7 @@ def test_optional_calls_a_loading_client_needs_no_lock(bound_opt, default_sock_l
         def env_for():
             env = fake_env(total_mib=200, ledger=tmp_path / "hbm",
                            extra={"NVSHARE_HOST_ARENA_MIB": 64, "NVSHARE_CHUNK_MIB": 8, "NVSHARE_BATCH_MIB": 32, "NVSHARE_DEBUG": 1})
-            env["LD_PRELOAD"] = str(bound_opt)
+            env["LD_PRELOAD"] = with_ref_shim(bound_opt)
             return env
         a = subprocess.Popen([str(ORACLE / "driver_app"), "40", "4.0", "1", "3"], env=env_for(),
                              stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True)

@@ -76,7 +76,7 @@ def test_uvm_mode_two_clients(artefacts, sock_dir, tmp_path):
 
 
 def test_gpu_without_our_kernel_image_runs_on_managed_memory(artefacts, sock_dir, tmp_path):
-    """ADVICE r1: only the sm_100a image is embedded; on any other GPU the drop-in must still work.  The engine
+    """ADVICE r1: only the sm_90a image is embedded; on any other GPU the drop-in must still work.  The engine
     fails to load its kernels, the library says so and runs the process on the reference's mechanism."""
     log, results = run_clients("ours", "ours", sock_dir, tmp_path, seconds=3.0, extra={"FAKE_CUDA_NO_BINARY": 1})
     check(results)

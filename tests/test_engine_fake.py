@@ -2,7 +2,7 @@
 (include/nvshare_engine.h), on CPU against oracle/fake_cuda.c.  The fake driver
 executes the copy kernels' byte semantics, so these tests cover descriptor
 generation, chunk state machine, LRU order, pools and error paths -- NOT the
-CUDA kernels themselves (tests/test_gpu_*.py do that on a B200).
+CUDA kernels themselves (tests/test_gpu_*.py do that on an H100).
 
 Checker: oracle/nvshare_oracle.c (liboracle.so) -- oracle_slab_move,
 oracle_pattern_*.
@@ -62,10 +62,10 @@ def view(ptr, nbytes):
 
 def test_version_and_default_config(fake):
     from nvshare_b200 import engine as E
-    assert b"sm_100a" in E.load().nvs_engine_version()
+    assert b"sm_90a" in E.load().nvs_engine_version()
     cfg = E.default_config()
     assert cfg.chunk_bytes == 256 * MiB and cfg.host_arena_bytes == 1024 * MiB
-    # pinned-host tier on the copy engines (256-byte TLPs), peer tier on the sm_100a kernel: engine.c, probes D/G
+    # pinned-host tier on the copy engines (256-byte TLPs), peer tier on the sm_90a kernel: engine.c, probes D/G
     assert cfg.evict_variant == E.COPY_CE and cfg.fetch_variant == E.COPY_CE
     assert cfg.peer_evict_variant == E.COPY_TMA and cfg.peer_fetch_variant == E.COPY_CE and cfg.retain == 1
     assert cfg.tma_stages == 6 and cfg.tma_tile_bytes == 32768 and cfg.tma_warps == 1
@@ -537,7 +537,7 @@ def test_best_effort_eviction_never_waits_for_backing_space(fake, tmp_path):
 
 
 def test_allocation_by_the_lock_holder_stops_waiting_when_the_lock_goes(fake, tmp_path):
-    """r2 call 5: the quantum ended while the holder's cuMemAlloc was waiting for HBM the other client still
+    """Seen with a ResNet-50 client: the quantum ended while the holder's cuMemAlloc was waiting for HBM the other client still
     had; the allocation kept the engine's entry lock for oom_wait_ms (120 s), the hand-off's eviction queued
     behind it, and the daemon rightly ignored pressure from a client that no longer held the lock.  Now the
     wait ends with the lock: what is mapped stays, the rest is virtual until the next fetch."""

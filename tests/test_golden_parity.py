@@ -1,6 +1,6 @@
 """Parity against the committed golden fixtures (tests/golden/*.json), which
 were recorded from the UNMODIFIED reference binaries by
-tests/golden/make_golden.py.  These tests need neither /root/reference nor
+tests/golden/make_golden.py.  These tests need neither the reference's sources nor
 oracle/_ref's reference build: only our own artefacts, the fake driver and the
 fixtures -- so they also run on the GPU box.
 
@@ -76,7 +76,7 @@ def test_ctl_frames_on_the_wire(artefacts, case, tmp_path):
 
 def test_hook_application_view_and_sync_pattern(artefacts, tmp_path):
     """Same application, our library: identical return codes, the 1536 MiB
-    reserve, the 100 GiB + 100 GiB -> OUT_OF_MEMORY cap, and the reference's
+    reserve, the 40 GiB + 40 GiB of 80 GiB -> OUT_OF_MEMORY cap, and the reference's
     launch / cuCtxSynchronize interleaving (window 1 -> 2 -> 4)."""
     gold = load("hook_golden.json")
     sock_dir = tmp_path / "nvs"; sock_dir.mkdir()

@@ -1,4 +1,4 @@
-"""LD_PRELOAD boundary on a real B200: unmodified PyTorch workloads
+"""LD_PRELOAD boundary on a real H100: unmodified PyTorch workloads
 (nvshare_b200/workloads.py, the restated tests/pytorch-add.py and
 tests/tf-matmul.py) run under OUR libnvshare.so + nvshare-scheduler, results
 checked exactly; plus a genuinely oversubscribed pair made possible on a small
@@ -95,24 +95,24 @@ def test_matmul_two_clients_within_tolerance(artefacts, tmp_path, pattern):
             assert moved >= 2 * 8192 * 8192 * 4                        # the operand and the product crossed the link
 
 
-def test_same_workload_under_the_reference_library_and_ours(artefacts, tmp_path, have_reference, default_sock_lock):
-    """The reference's libnvshare.so + nvshare-scheduler (oracle/_ref, unmodified: cuMemAllocManaged and
-    UVM faults) and ours run the same seeded workloads on the same GPU; each verifies its own results
-    and prints checksums of its output tensor, which must be identical between the two."""
-    if not have_reference:
-        pytest.skip("compiled reference (oracle/_ref) not available")
-    from nvs_testlib import ORACLE
+def test_same_workload_under_the_reference_library_and_ours(artefacts, tmp_path, have_reference, request):
+    """Ours and -- where it can run -- the reference's libnvshare.so + nvshare-scheduler (oracle/_ref,
+    unmodified: cuMemAllocManaged and UVM faults) run the same seeded workloads on the same GPU; each
+    verifies its own results and prints checksums of its output tensor, which must be identical to
+    those of the un-hooked application (tests/golden/workload_checksums.json, make_golden.py)."""
+    sys.path.insert(0, str(ROOT / "tests" / "golden"))
+    from make_golden import CHECKSUM_WORKLOADS
+    gold = json.loads((ROOT / "tests" / "golden" / "workload_checksums.json").read_text())
     sums = {}
-    for arm in ("reference", "ours"):
-        sock_dir = default_sock_lock if arm == "reference" else tmp_path / "nvs"
+    for arm in (("reference", "ours") if have_reference else ("ours",)):
+        sock_dir = request.getfixturevalue("default_sock_lock") if arm == "reference" else tmp_path / "nvs"
         sock_dir.mkdir(exist_ok=True)
         d = Daemon(arm, sock_dir, log_path=tmp_path / f"sched_{arm}.log")
         try:
             d.ctl("-T", "2", impl=arm)
             procs = []
-            for i, (kind, n) in enumerate((("add", 12000), ("matmul", 6144))):
-                lib = str(ORACLE / "libnvshare.so") if arm == "reference" else preload("ours")
-                env = dict(os.environ, LD_PRELOAD=lib, PYTHONPATH=str(ROOT), NVSHARE_EVICT_POLICY="all")
+            for i, (kind, n) in enumerate(CHECKSUM_WORKLOADS):
+                env = dict(os.environ, LD_PRELOAD=preload(arm), PYTHONPATH=str(ROOT), NVSHARE_EVICT_POLICY="all")
                 if arm == "ours":
                     env["NVSHARE_SOCK_DIR"] = str(sock_dir)
                 procs.append(subprocess.Popen(client_cmd(kind, n, 6, "pos", tmp_path / f"{arm}{i}.jsonl", f"{arm}{i}"),
@@ -121,11 +121,12 @@ def test_same_workload_under_the_reference_library_and_ours(artefacts, tmp_path,
                 out, err = p.communicate(timeout=900)
                 assert p.returncode == 0 and out.startswith("PASS"), arm + out + err[-3000:]
                 summary = json.loads(out.splitlines()[0].split(" ", 1)[1])
-                sums[(arm, i)] = (summary["z_sum"], summary["z_wsum"])
+                sums[(arm, i)] = [summary["z_sum"], summary["z_wsum"]]
         finally:
             d.stop()
-    for i in (0, 1):
-        assert sums[("reference", i)] == sums[("ours", i)], sums
+    for (arm, i), got in sums.items():
+        kind, n = CHECKSUM_WORKLOADS[i]
+        assert got == gold[f"{kind}_{n}"], (arm, kind, got)
 
 
 def test_oversubscribed_pair_with_ballast(artefacts, tmp_path):

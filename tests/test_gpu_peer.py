@@ -24,7 +24,7 @@ def torch2():
 
 @pytest.mark.parametrize("fetch_v", ["tma", "ce"])
 def test_evict_to_peer_hbm_and_back(torch2, artefacts, fetch_v):
-    """Eviction always on the sm_100a TMA kernel; the fetch on the kernel (a fetch that has the GPU to itself)
+    """Eviction always on the sm_90a TMA kernel; the fetch on the kernel (a fetch that has the GPU to itself)
     and on the copy engines (the default: it overlaps the previous holder's eviction kernel)."""
     torch = torch2
     from nvshare_b200 import engine as E

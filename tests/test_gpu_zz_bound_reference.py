@@ -15,7 +15,7 @@ import subprocess
 
 import pytest
 
-from nvs_testlib import ORACLE, Daemon
+from nvs_testlib import ORACLE, Daemon, with_ref_shim
 
 pytestmark = [pytest.mark.gpu, pytest.mark.reference]
 BOUND = ORACLE / "libnvshare_bound.so"
@@ -29,7 +29,7 @@ def test_reference_hook_and_client_over_our_engine_on_the_gpu(artefacts, default
         procs = []
         d.ctl("-T", "1")
         for i in (1, 2):
-            env = dict(os.environ, LD_PRELOAD=str(BOUND), NVSHARE_DEBUG="1", DRIVER_APP_NO_LAUNCH="1",
+            env = dict(os.environ, LD_PRELOAD=with_ref_shim(BOUND), NVSHARE_DEBUG="1", DRIVER_APP_NO_LAUNCH="1",
                        NVSHARE_STATS_FILE=str(tmp_path / f"stats{i}.jsonl"))
             procs.append(subprocess.Popen([str(ORACLE / "driver_app"), "256", "6.0", str(i), "3"], env=env,
                                           stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True))

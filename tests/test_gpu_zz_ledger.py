@@ -1,9 +1,8 @@
 """The GPU ledger (nvshare_b200/csrc/gpu_ledger.c) on the real driver.  Its rules are pinned on the fake
-driver's four GPUs (test_gpu_ledger_fake.py); here: that the ledger comes up on a B200 at all (the UUID and
+driver's four GPUs (test_gpu_ledger_fake.py); here: that the ledger comes up on an H100 at all (the UUID and
 the total come from the driver), that the engine's own footprint is on record where other processes can see
 it and leaves with the memory, and -- on a box with two GPUs -- that what an engine backs on GPU 1 is
-accounted on GPU 1 while it is there.  (This file sorts last on purpose: it was written after the round's GPU
-minutes were spent and ran by hand once, profiles/r02_call12_ledger_on_b200.txt.)"""
+accounted on GPU 1 while it is there."""
 from __future__ import annotations
 
 import pytest

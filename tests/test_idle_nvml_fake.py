@@ -40,7 +40,7 @@ def run_idle_client(sock_dir, tmp_path, util, extra=None):
 def test_idle_client_on_gpu1_releases_although_gpu0_is_busy(artefacts, sock_dir, tmp_path):
     err, trace = run_idle_client(sock_dir, tmp_path, "100,0")           # physical GPU 0 busy, GPU 1 (ours) idle
     assert "Found NVML" in err
-    h = (b"GPU-FAKE-B200-" + bytes([0, 1])).hex()                        # the fake driver's UUID of physical GPU 1
+    h = (b"GPU-FAKE-H100-" + bytes([0, 1])).hex()                        # the fake driver's UUID of physical GPU 1
     assert f"Early release watches the utilisation of GPU-{h[:8]}-{h[8:12]}-{h[12:16]}-{h[16:20]}-{h[20:]} (CUDA device 1)" in err
     assert "by_uuid 1" in trace and "util 1" in trace and "util 0" not in trace
     assert "Releasing the lock early due to inactivity" in err

@@ -147,7 +147,7 @@ def test_reference_daemon_gets_the_conservative_policy(artefacts, default_sock_l
                            extra={"NVSHARE_HOST_ARENA_MIB": 64, "NVSHARE_CHUNK_MIB": 8, "NVSHARE_DEBUG": 1,
                                   "NVSHARE_POOL_GIB": 1, "NVSHARE_STATS_FILE": tmp_path / f"stats{i}.jsonl"})
             env["LD_PRELOAD"] = preload("ours")
-            env.pop("NVSHARE_SOCK_DIR", None)
+            env["NVSHARE_SOCK_DIR"] = str(default_sock_lock)
             procs.append(subprocess.Popen([str(ORACLE / "driver_app"), "80", "4", str(i), "3"], env=env,
                                           stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True))
         finish(procs)

@@ -1,7 +1,7 @@
 """Clean-slab skip (SURVEY 8f rank 3, "pre-cleaning"): backing copies are kept
 after a fetch, every slab's 128-bit content hash is recorded when its copy is
 written, and the next eviction copies only slabs whose hash changed.  CPU, fake
-driver (which computes the same hash as the sm_100a scan kernel through
+driver (which computes the same hash as the sm_90a scan kernel through
 oracle/slab_hash_ref.h); the kernel itself is checked against the oracle on the
 GPU (tests/test_gpu_engine.py)."""
 from __future__ import annotations

@@ -3,18 +3,23 @@ actions (register, request, release, disconnect, nvsharectl-style status/TQ
 messages, malformed frames) is applied to the REFERENCE nvshare-scheduler and to
 ours; every client's received message-type sequence must be identical.  The time
 quantum is set to an hour so that only message-driven transitions occur (the
-timer path is covered with real time in test_scheduler_protocol.py)."""
+timer path is covered with real time in test_scheduler_protocol.py).  What the
+reference daemon did with each script is stored in
+tests/golden/scheduler_differential_golden.json (tests/golden/make_golden.py)."""
 from __future__ import annotations
 
+import json
 import random
 import time
+from pathlib import Path
 
 import pytest
 
 from nvs_testlib import (LOCK_RELEASED, REGISTER, REQ_LOCK, SCHED_OFF, SCHED_ON, SET_TQ, TYPE_NAMES, Daemon,
                          MockClient, pack)
 
-pytestmark = pytest.mark.reference
+GOLDEN = Path(__file__).resolve().parent / "golden" / "scheduler_differential_golden.json"
+SEEDS = range(12)
 
 
 def run_script(d, seed, n_clients=4, n_ops=60):
@@ -95,13 +100,10 @@ def run_script(d, seed, n_clients=4, n_ops=60):
     return trace, log
 
 
-@pytest.mark.parametrize("seed", range(12))
-def test_same_script_same_trace(artefacts, default_sock_lock, tmp_path, seed):
-    ref = Daemon("reference", default_sock_lock)
-    try:
-        want, log = run_script(ref, seed)
-    finally:
-        ref.stop()
+@pytest.mark.parametrize("seed", SEEDS)
+def test_same_script_same_trace(artefacts, tmp_path, seed):
+    gold = {g["seed"]: g for g in json.loads(GOLDEN.read_text())}[seed]
+    want, log = gold["trace"], [tuple(x) for x in gold["script"]]
     sock_dir = tmp_path / "nvs"
     sock_dir.mkdir()
     ours = Daemon("ours", sock_dir)

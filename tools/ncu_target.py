@@ -1,7 +1,7 @@
 """Short, deterministic exercise of the copy kernels for profiling under ncu:
   1. eviction of 4 GiB to pinned host memory  (nvs_slab_copy_tma, 8 CTAs, PCIe-bound)
   2. fetch of the same with the TMA variant    (host -> HBM)
-  3. a device-to-device pass over 4 GiB        (nvs_slab_copy_tma, 148 CTAs, HBM-bound)
+  3. a device-to-device pass over 4 GiB        (nvs_slab_copy_tma, one CTA per SM, HBM-bound)
   4. scan + splat of same-filled data          (nvs_slab_scan / nvs_slab_splat)
 Numbers printed here are taken under a profiler and are NOT bench values."""
 import sys
@@ -23,7 +23,7 @@ with E.Engine(fetch_variant="tma", shared_pool_path=None) as e:
     print("fetch", e.fetch_all())
     q = e.alloc(size)
     e.fetch_all()
-    ms = e.copy_slabs([(p + o, q + o, 2 * MiB) for o in range(0, size, 2 * MiB)], variant="tma", grid=148)
+    ms = e.copy_slabs([(p + o, q + o, 2 * MiB) for o in range(0, size, 2 * MiB)], variant="tma", grid=torch.cuda.get_device_properties(0).multi_processor_count)
     print("d2d ms", ms, "GB/s payload", size / 1e6 / ms)
     t = torch.empty(1, device="cuda")
     e.free(q)

@@ -1,8 +1,8 @@
-"""Round 2: short, deterministic exercise of the sm_100a kernels for profiling under ncu:
+"""Round 2: short, deterministic exercise of the sm_90a kernels for profiling under ncu:
   1. eviction of 4 GiB of position-dependent data: nvs_slab_scan (hash mode, one launch over 2048 slabs,
      HBM-bound) + copy engines; fetch; a second eviction that finds everything clean (scan only)
-  2. a device-to-device pass over 4 GiB (nvs_slab_copy_tma, 148 CTAs, HBM-bound)
-  3. with --peer: eviction / fetch of 4 GiB to the HBM of GPU 1 (nvs_slab_copy_tma over NVLink, 74 CTAs)
+  2. a device-to-device pass over 4 GiB (nvs_slab_copy_tma, one CTA per SM, HBM-bound)
+  3. with --peer: eviction / fetch of 4 GiB to the HBM of GPU 1 (nvs_slab_copy_tma over NVLink, half the SMs)
   4. scan + splat of same-filled data (nvs_slab_scan quick mode / nvs_slab_splat)
 Numbers printed here are taken under a profiler and are NOT bench values."""
 import sys
@@ -30,7 +30,7 @@ with E.Engine(**kw) as e:
     print("fetch", e.fetch_all())
     q = e.alloc(size)
     e.fetch_all()
-    ms = e.copy_slabs([(p + o, q + o, 2 * MiB) for o in range(0, size, 2 * MiB)], variant="tma", grid=148)
+    ms = e.copy_slabs([(p + o, q + o, 2 * MiB) for o in range(0, size, 2 * MiB)], variant="tma", grid=torch.cuda.get_device_properties(0).multi_processor_count)
     print("d2d ms", ms, "GB/s payload", size / 1e6 / ms)
     e.free(q)
 

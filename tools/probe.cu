@@ -1,5 +1,5 @@
 /*
- * probe.cu -- one-shot measurement of every B200 / driver constant the swap
+ * probe.cu -- one-shot measurement of every GPU / driver constant the swap
  * engine's design depends on (DESIGN.md cites the numbers this prints):
  *
  *   A  device + host facts (SMs, HBM, VMM granularity, host RAM, cores)
@@ -15,7 +15,7 @@
  *   F  peer-HBM tier (only when >= 2 devices are visible)
  *
  * Output: one JSON object per line on stdout ("PROBE {...}").
- * Build:  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo \
+ * Build:  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo \
  *              -o tools/probe tools/probe.cu -lcuda
  * This is a measurement tool, not part of the product path.
  */
@@ -502,7 +502,7 @@ static int section_d(void)
 	}
 
 	/* 2. TMA sweep */
-	const int grids[] = {1, 2, 4, 8, 16, 32, 74, 148};
+	const int grids[] = {1, 2, 4, 8, 16, 32, 66, 132};
 	const Geo shapes[] = {
 		{NVS_COPY_TMA, 0, 1, 6, 32768},
 		{NVS_COPY_TMA, 0, 4, 3, 16384},
@@ -514,7 +514,7 @@ static int section_d(void)
 		for (int grid : grids) {
 			Geo g = sh;
 			g.grid = grid;
-			bool check = (grid == 8 || grid == 148);
+			bool check = (grid == 8 || grid == 132);
 			if (run_case(b, "d2h", g, false, check)) return -1;
 			if (run_case(b, "h2d", g, false, check)) return -1;
 			if (grid >= 2) {
@@ -530,7 +530,7 @@ static int section_d(void)
 	for (int warps : {8, 16}) {
 		for (int grid : grids) {
 			Geo g = {NVS_COPY_LDG, grid, warps, 0, 0};
-			bool check = (grid == 8 || grid == 148);
+			bool check = (grid == 8 || grid == 132);
 			if (run_case(b, "d2h", g, false, check)) return -1;
 			if (run_case(b, "h2d", g, false, check)) return -1;
 			if (grid >= 2) {
@@ -684,7 +684,7 @@ static int section_f(void)
 	RT(cudaFuncSetAttribute(nvs_slab_copy_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
 	if (fill(b, b.dev_a, 1))
 		return -1;
-	const int grids[] = {8, 16, 32, 74, 148};
+	const int grids[] = {8, 16, 32, 66, 132};
 	for (int pass = 0; pass < 2; ++pass) {
 		/* pass 0: local -> peer (evict); pass 1: peer -> local (fetch) */
 		if (pass == 1) {
@@ -697,11 +697,11 @@ static int section_f(void)
 		if (run_case(b, "d2d", ce, false, true)) return -1;
 		for (int grid : grids) {
 			Geo t = {NVS_COPY_TMA, grid, 1, 6, 32768};
-			if (run_case(b, "d2d", t, false, grid == 148)) return -1;
+			if (run_case(b, "d2d", t, false, grid == 132)) return -1;
 			Geo t2 = {NVS_COPY_TMA, grid, 4, 3, 16384};
-			if (run_case(b, "d2d", t2, false, grid == 148)) return -1;
+			if (run_case(b, "d2d", t2, false, grid == 132)) return -1;
 			Geo l = {NVS_COPY_LDG, grid, 8, 0, 0};
-			if (run_case(b, "d2d", l, false, grid == 148)) return -1;
+			if (run_case(b, "d2d", l, false, grid == 132)) return -1;
 		}
 	}
 	return 0;
@@ -878,8 +878,8 @@ static int section_h(void)
 }
 
 /* --------------------------------------------------------------- J ------ */
-/* Why do cuMemUnmap + cuMemRelease cost ~8 ms per 256 MiB chunk inside a real
- * hand-off (r01 call 3) when section B measured 0.14 ms?  Time them separately:
+/* Why can cuMemUnmap + cuMemRelease cost far more per 256 MiB chunk inside a real
+ * hand-off than section B measures?  Time them separately:
  * idle, beside our own copy kernel, beside another process's copy-engine traffic,
  * and with one cuMemUnmap spanning several chunks. */
 struct JState {
@@ -1071,8 +1071,8 @@ static int section_j_two_process(void)
 /* The hand-off with HBM FULL: process A owns ~all free HBM in 256 MiB chunks and
  * gives it back chunk by chunk (unmap + release); process B grabs whatever
  * becomes free (create + map + setaccess), exactly like evict vs fetch but with
- * no data movement.  r01 call 4 saw ~7.5 ms per chunk in the real hand-off
- * against 0.4 ms in section J (where HBM was never short).  Variants:
+ * no data movement: a real hand-off can see per-chunk costs far above those of
+ * section J (where HBM is never short).  Variants:
  *   mode 0  B polls cuMemGetInfo every 1 ms and maps as soon as one chunk fits
  *   mode 1  B maps only when >= 8 GiB are free (A runs ahead, calls interleave less)
  *   mode 2  B does not run at all (A alone, memory full at start)            */
