@@ -278,7 +278,12 @@ typedef struct nvs_scan_out {
 	uint64_t is_const; /* 1: every 64-bit word of the slab equals `value`               */
 	uint64_t h0, h1;   /* 128-bit content hash (0, 0 when not asked for)                */
 } nvs_scan_out;
-/* Run the scan/hash kernel over descs[i].src / .bytes (dst ignored); out[n]. */
+/* Run the scan/hash kernel over descs[i].src / .bytes; out[n].  descs[i].dst == 0: scan only; with
+ * want_hash == 0 the scan may stop at the first 32 KiB tile that differs and reports no hash.
+ * descs[i].dst != 0: fused copy + hash, as the background pre-cleaner runs it: [src, src+bytes) is
+ * copied to dst in full, and the hash is reported whatever want_hash says and describes the bytes
+ * that landed in dst.  src, dst and bytes must be multiples of 16 (else NVS_E_BAD_ARG, nothing
+ * launched), bytes > 0. */
 int nvs_scan_slabs(nvs_engine *e, const nvs_copy_desc *descs, uint32_t n, int want_hash, nvs_scan_out *out,
 		   float *ms);
 int nvs_pattern_fill(nvs_engine *e, uint64_t addr, uint64_t n_words, uint64_t first_index, uint64_t seed);

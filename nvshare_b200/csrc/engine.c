@@ -3331,8 +3331,9 @@ int nvs_scan_slabs(nvs_engine *e, const nvs_copy_desc *descs, uint32_t n, int wa
 {
 	if (!e || (!descs && n) || (!out && n))
 		return NVS_E_BAD_ARG;
+	/* dst != 0: the fused copy + hash the pre-cleaner uses; the kernel stores 16-byte vectors to it */
 	for (uint32_t i = 0; i < n; ++i)
-		if ((descs[i].src & 15ull) || (descs[i].bytes & 15ull) || descs[i].bytes == 0)
+		if (((descs[i].src | descs[i].dst) & 15ull) || (descs[i].bytes & 15ull) || descs[i].bytes == 0)
 			return NVS_E_BAD_ARG;
 	if (n == 0)
 		return 0;

@@ -247,12 +247,16 @@ class Engine:
         return bad.value
 
 
-def scan_slabs(engine: Engine, descs, want_hash=True, with_ms=False):
-    """nvs_scan_slabs: run the sm_90a scan/hash kernel over (src, _, nbytes) ranges."""
+def scan_slabs(engine: Engine, descs, want_hash=True, with_ms=False, copy=False):
+    """nvs_scan_slabs: run the sm_90a scan/hash kernel over (src, dst, nbytes) ranges.
+
+    copy=False scans only: dst is not passed on, so copy descriptors can be reused to scan their sources.
+    copy=True passes dst through: a non-zero dst makes that range a fused copy + hash (copied in full, always
+    hashed, the hash describing the bytes that landed in dst)."""
     descs = list(descs)
     arr = (CopyDesc * max(len(descs), 1))()
-    for i, (s, _d, b) in enumerate(descs):
-        arr[i].src, arr[i].dst, arr[i].bytes, arr[i].tag = s, 0, b, i
+    for i, (s, d, b) in enumerate(descs):
+        arr[i].src, arr[i].dst, arr[i].bytes, arr[i].tag = s, d if copy else 0, b, i
     out = (ScanOut * max(len(descs), 1))()
     ms = C.c_float()
     _check(load().nvs_scan_slabs(engine._h, arr, len(descs), 1 if want_hash else 0, out, C.byref(ms)), "nvs_scan_slabs")

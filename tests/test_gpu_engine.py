@@ -303,6 +303,9 @@ def test_background_precleaning_with_the_fused_copy_hash_kernel(torch_cuda, arte
         quiet, busy = e.alloc(size), e.alloc(size)
         e.fetch_all()
         e.pattern_fill(quiet, size // 8, first_index=3, seed=8)
+        # fetch_all already puts the engine in resident mode: chunks the pre-cleaner wrote back before this fill
+        # hold the old contents and are copied again.  It goes in allocation order, so they are `quiet`'s first ones.
+        stale = e.stats()["precleaned_bytes_total"]
 
         class Raw:
             def __init__(self, ptr, n):
@@ -320,7 +323,7 @@ def test_background_precleaning_with_the_fused_copy_hash_kernel(torch_cuda, arte
         torch.cuda.synchronize()
         added = int(t[0].item())
         r = e.evict(0)
-        assert r["clean_bytes"] >= size and r["bytes"] + r["clean_bytes"] + r["elided_bytes"] == 2 * size   # `quiet` was not copied again
+        assert r["clean_bytes"] >= size - min(stale, size) and r["bytes"] + r["clean_bytes"] + r["elided_bytes"] == 2 * size   # `quiet` was not copied again
         assert r["bytes"] > 0                                                                            # `busy` had changed
         e.fetch_all()
         assert e.pattern_verify(quiet, size // 8, first_index=3, seed=8) == 0
